@@ -82,6 +82,17 @@ int sdet_roi_align_v2_backward(const float* ograd, const float* argmax_x, const 
                                float* grad_data, float* grad_rois, int B, int N, int C, int H,
                                int W, int pooled_h, int pooled_w, int accumulate, void* stream);
 
+/* Deterministic backward, same arguments.  Returns bit for bit the reference's backward run serially: per gradient
+ * plane, kWriteTo starts from +0.0 (kAddTo from the existing value) and the contributions are added with
+ * round-to-nearest fadd in ascending index ((n*C + c)*PH + ph)*PW + pw, each index adding its corners TL, TR, BL, BR
+ * as separate adds ((ograd * wy) * wx, rounded product by product); argmax -1 entries add nothing.  No global
+ * atomics, no allocation, no host synchronisation.  Every check happens before the first launch or memset; on an
+ * error nothing is launched and the outputs are untouched.  SDET_ERR_UNSUPPORTED: W > 12288 (a plane row must fit
+ * one shared-memory band) or pooled_size > SDET_MAX_POOLED.  torch's deterministic mode selects it (ops.py). */
+int sdet_roi_align_v2_backward_ordered(const float* ograd, const float* argmax_x, const float* argmax_y,
+                                       float* grad_data, float* grad_rois, int B, int N, int C, int H,
+                                       int W, int pooled_h, int pooled_w, int accumulate, void* stream);
+
 /* Fused FPN RoIAlign: replaces  assign_layer_fpn (models/FPN/assign_layer_fpn.py:17-40) /
  * mxnext.tvm.fpn_roi_assign  +  num_levels x _contrib_ROIAlign_v2  +  add_n
  * (models/FPN/builder.py:573-605).  Each roi is sampled on its assigned level only; the result
@@ -133,9 +144,16 @@ int sdet_fpn_roi_align_v2_backward(const float* ograd, const float* argmax_x,
                                    float* const* grad_feats, const int* H, const int* W,
                                    int num_levels, int B, int N, int C, int pooled_h, int pooled_w,
                                    int accumulate, void* stream);
+/* Deterministic backward of the fused op, same arguments: per level l, the serial loop of
+ * sdet_roi_align_v2_backward_ordered over the rois with levels[n] == l (rois with level -1 add nothing). */
+int sdet_fpn_roi_align_v2_backward_ordered(const float* ograd, const float* argmax_x,
+                                           const float* argmax_y, const int32_t* levels,
+                                           float* const* grad_feats, const int* H, const int* W,
+                                           int num_levels, int B, int N, int C, int pooled_h, int pooled_w,
+                                           int accumulate, void* stream);
 
 /* ------------------------------------------------------------------------------------------
- * ROIPooling_v1   (operator_cxx/roi_pooling_v1.cc:243, op roi_pooling_v1-inl.h:63-137,
+ * ROIPooling_v1  (operator_cxx/roi_pooling_v1.cc:243, op roi_pooling_v1-inl.h:63-137,
  *                  kernels roi_pooling_v1.cu:49-113 / :116-152)
  *   data (B,C,H,W), rois (R,5) = [batch_index,x1,y1,x2,y2]; out, max_idx (R,C,PH,PW);
  *   max_idx holds the flat h*W+w index as float, -1 for empty bins.
@@ -149,6 +167,14 @@ int sdet_roi_pooling_v1_backward(const float* ograd, const float* max_idx, const
                                  float* grad_data, float* grad_rois, int B, int R, int C, int H,
                                  int W, int pooled_h, int pooled_w, float spatial_scale, int accumulate,
                                  void* stream);
+/* Deterministic backward, same arguments: per gradient plane, ograd[index] is added at max_idx[index] of image
+ * (int)rois[n*5] in ascending index ((n*C + c)*PH + ph)*PW + pw, from +0.0 on kWriteTo.  Entries with max_idx -1
+ * (or outside [0, H*W)) or an image index outside [0, B) add nothing; spatial_scale is not used.  Checks, errors
+ * and limits as sdet_roi_align_v2_backward_ordered. */
+int sdet_roi_pooling_v1_backward_ordered(const float* ograd, const float* max_idx, const float* rois,
+                                         float* grad_data, float* grad_rois, int B, int R, int C, int H,
+                                         int W, int pooled_h, int pooled_w, float spatial_scale,
+                                         int accumulate, void* stream);
 
 
 /* ------------------------------------------------------------------------------------------

@@ -51,6 +51,12 @@ _SIGNATURES = {
                                     c_int, c_float, _P],
     "sdet_roi_pooling_v1_backward": [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_float, c_int, _P],
+    "sdet_roi_align_v2_backward_ordered": [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
+                                           c_int, c_int, _P],
+    "sdet_fpn_roi_align_v2_backward_ordered": [_P, _P, _P, _P, POINTER(_P), POINTER(c_int), POINTER(c_int),
+                                               c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P],
+    "sdet_roi_pooling_v1_backward_ordered": [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int,
+                                             c_int, c_float, c_int, _P],
     "sdet_decode_bbox": [_P, _P, _P, _P, c_int, c_int, c_int, POINTER(c_float), POINTER(c_float), c_int,
                          c_int, _P],
     "sdet_proposal_v3_workspace": [c_int, c_int, c_int, c_int, c_int],

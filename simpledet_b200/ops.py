@@ -113,6 +113,15 @@ def roi_align_v2_raw(data, rois, pooled_size, spatial_scale, with_argmax=True, u
     return out, ax, ay
 
 
+def _backward_entry(name: str):
+    """The RoI pooling backward entry `name`, or its `_ordered` twin under torch.use_deterministic_algorithms(True):
+    the default entries scatter with float atomics, the ordered ones return the serial sum in index order, bit for bit
+    the same on every run."""
+    if torch.are_deterministic_algorithms_enabled():
+        name += "_ordered"
+    return getattr(_lib.lib(), name)
+
+
 class _ROIAlignV2Fn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, data, rois, ph, pw, spatial_scale):
@@ -134,8 +143,8 @@ class _ROIAlignV2Fn(torch.autograd.Function):
         ograd = _dev(ograd, "ograd")
         grad = torch.empty(ctx.dshape, device=ograd.device, dtype=torch.float32)
         ph, pw = ograd.shape[3], ograd.shape[4]
-        check(_lib.lib().sdet_roi_align_v2_backward(_p(ograd), _p(ax), _p(ay), _p(grad), None, B, N,
-                                                    C, H, W, ph, pw, 0, _stream()))
+        check(_backward_entry("sdet_roi_align_v2_backward")(_p(ograd), _p(ax), _p(ay), _p(grad), None, B, N,
+                                                            C, H, W, ph, pw, 0, _stream()))
         # grad_rois is identically zero in the reference (roi_align_v2.cu:139-141)
         return grad, None, None, None, None
 
@@ -259,7 +268,7 @@ class _FpnRoiAlignFn(torch.autograd.Function):
         ptrs = (ctypes.c_void_p * L)(*[g.data_ptr() for g in grads])
         Hs = (ctypes.c_int * L)(*[s[2] for s in ctx.shapes])
         Ws = (ctypes.c_int * L)(*[s[3] for s in ctx.shapes])
-        check(_lib.lib().sdet_fpn_roi_align_v2_backward(
+        check(_backward_entry("sdet_fpn_roi_align_v2_backward")(
             _p(ograd), _p(ax), _p(ay), _p(levels), ptrs, Hs, Ws, L, B, ctx.N, C, ograd.shape[3],
             ograd.shape[4], 0, _stream()))
         return (None, None, None, None, None, None, *grads)
@@ -433,8 +442,8 @@ class _ROIPoolingV1Fn(torch.autograd.Function):
         ograd = _dev(ograd, "ograd")
         R, _, ph, pw = ograd.shape
         grad = torch.empty(ctx.dshape, device=ograd.device, dtype=torch.float32)
-        check(_lib.lib().sdet_roi_pooling_v1_backward(_p(ograd), _p(idx), _p(rois), _p(grad), None, B,
-                                                      R, C, H, W, ph, pw, ctx.scale, 0, _stream()))
+        check(_backward_entry("sdet_roi_pooling_v1_backward")(_p(ograd), _p(idx), _p(rois), _p(grad), None, B,
+                                                              R, C, H, W, ph, pw, ctx.scale, 0, _stream()))
         return grad, None, None, None, None
 
 
